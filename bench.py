@@ -43,7 +43,7 @@ def parse():
                     help="ptv3_base = the headline metric (BASELINE config 4 shape); spunet34 = BASELINE config 3 (supplementary)")
     ap.add_argument("--fused-linear", action="store_true", help="fused bias-gradient Linear (pays off for GPU-bound batches)")
     ap.add_argument("--no-reorder", action="store_true", help="keep level-0 points in input order (no z-order memory layout)")
-    ap.add_argument("--kernel-impl", type=int, default=None, help="0 auto, 1 SIMT kernels, 2 tcgen05 kernels")
+    ap.add_argument("--kernel-impl", type=int, default=None, help="0 auto, 1 SIMT kernels, 2 tensor-core kernels")
     ap.add_argument("--no-supplementary", action="store_true", help="skip the short BASELINE config 3 / config 5 runs")
     ap.add_argument("--no-gpu-reference", action="store_true", help="skip the BASELINE.md B2 comparator (stock flash-attn + torch conv)")
     ap.add_argument("--gpu-reference-steps", type=int, default=5)
@@ -58,6 +58,9 @@ def parse():
                     help="N = 1 only: initialise NCCL with world size 1 and run the gradient exchange anyway (measures its overhead)")
     ap.add_argument("--torch-profile", default=None, help="write a torch.profiler (CUPTI) per-kernel breakdown of two extra steps to this file")
     ap.add_argument("--torch-adamw", action="store_true", help="torch.optim.AdamW(fused=True) instead of pointcept_b200.optim.FusedAdamW")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (rank 0) as DIR/<name>.npy: seg_logits, loss and a "
+                         "fixed, seeded sample of the parameter gradients (float32, < 64 MB in all), to compare two builds output for output")
     return ap.parse_args()
 
 
@@ -93,7 +96,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, source="fallback")
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=989.0, source="H100 SXM data sheet (dense bf16, 700 W), not measured")
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -207,9 +210,9 @@ def run_reference(args):
 # GPU arm
 # ---------------------------------------------------------------------------------------------------------
 ATTAINABLE = {  # structural ceilings of the D = 16 attention kernels as a fraction of the tensor peak (DESIGN.md section 4)
-    "attn_fwd": "exp pipe: 64 MMA-flop per ex2 at 16 ex2/clk/SM caps the forward near 0.20 of the bf16 tensor peak",
-    "attn_bwd": "160 MMA-flop per ex2 and 8 B of TMEM reads per score cap the backward near 0.5 of the tensor peak; the measured limiter is "
-                "the issue cadence of its small MMAs (~36 TC-pipe cycles per tcgen05.mma, profiles/r02_ncu_attn_bwd_bq32_ring4_full_metrics.txt)",
+    "attn_fwd": "exp pipe: 64 MMA-flop per ex2 at 16 ex2/clk/SM (132 SMs, 1.98 GHz) caps the forward near 0.27 of the dense bf16 tensor peak",
+    "attn_bwd": "160 MMA-flop per score and two ex2 per score (dK/dV and dQ kernels each form P) at 16 ex2/clk/SM cap the backward "
+                "near 0.34 of the dense bf16 tensor peak",
 }
 
 
@@ -283,10 +286,14 @@ def measure(args, workload, scenes, voxels, steps, warmup, kind="indoor", want_p
         d["offset_host"], d["grid_max_host"] = offset_host, grid_max_host   # host metadata the collate already has
         return d
 
+    last = {}
+
     def step(d):
         opt.zero_grad(set_to_none=True)
         with torch.autocast("cuda", dtype=torch.bfloat16):
             out = net(d)
+        if args.dump_outputs:
+            last["out"] = out
         out["loss"].backward()
         if reducer is not None:
             reducer.finish()
@@ -361,6 +368,9 @@ def measure(args, workload, scenes, voxels, steps, warmup, kind="indoor", want_p
             dist.all_reduce(pts, op=dist.ReduceOp.SUM)
         total_points = float(pts.item())
         res.update(total_points=total_points, ms_per_step=ms_total / steps, value=total_points * steps / (ms_total * 1e-3))
+        if args.dump_outputs and want_profile and rank == 0:
+            dump_outputs(args.dump_outputs, last["out"], model)
+        last.clear()
         # ---- roofline leg: the same steps, same (compiled) binding, with the library's own event pair around every hot entry
         # point (b2pc_profile_*); kept out of region 1 so that the event bookkeeping does not tax the headline number
         if want_profile:
@@ -415,16 +425,25 @@ def measure(args, workload, scenes, voxels, steps, warmup, kind="indoor", want_p
     return res
 
 
+def dump_outputs(out_dir, out, model, grad_sample=1 << 20):
+    """What the last timed step computed: the segmentation logits and loss the forward returned and, of the parameter gradients
+    (all of them together are larger than the 64 MB budget), the `grad_sample` entries of their concatenation in named_parameters()
+    order at the sorted positions torch.randperm(n, generator=torch.Generator().manual_seed(0))[:grad_sample] picks.  The parameter
+    update of that step is not included."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "seg_logits.npy"), out["seg_logits"].detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "loss.npy"), out["loss"].detach().float().cpu().numpy().reshape(1))
+    grads = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach().float().reshape(-1) for _, p in model.named_parameters()])
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randperm(grads.numel(), generator=g)[:grad_sample].sort().values
+    np.save(os.path.join(out_dir, "grad_sample.npy"), grads[idx.to(grads.device)].cpu().numpy())
+
+
 def rooflines(prof, prof_ms_total, pk):
     """per entry point: achieved algorithmic rate against the bound that applies (SURVEY.md 8(d)) -> (list, shares)"""
     out, shares = [], {}
-    traffic = {}
-    tpath = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if os.path.exists(tpath):
-        try:
-            traffic = {k: v for k, v in json.load(open(tpath)).items() if not k.startswith("_")}
-        except Exception:
-            traffic = {}
     for name, r in prof.items():
         shares[name] = round(r["ms"] / prof_ms_total, 4)
         if r["ms"] <= 0:
@@ -440,7 +459,6 @@ def rooflines(prof, prof_ms_total, pk):
             ent.update(bound="hbm", achieved=ach, peak=pk["hbm"], unit="GB/s", frac=ach / pk["hbm"], peak_source=pk["source"] + " (copy)")
         else:
             continue
-        ent["traffic"] = traffic.get(name)
         out.append(ent)
     out.sort(key=lambda e: -e["share_of_step"])
     return out, shares
@@ -495,7 +513,7 @@ def run_ours(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 operators have no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device -- the CUDA operators have no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1 or args.force_dist:
@@ -578,7 +596,7 @@ def run_ours(args):
                    "scenes_per_gpu": args.scenes_per_gpu, "points_per_gpu": main["points_per_gpu"], "global_points": int(main["total_points"]),
                    "params_M": main["params_M"], "patch_size": 1024, "orders": 4, "parallelism": f"dp{world}",
                    "grad_exchange": main.get("grad_exchange"),
-                   "l2": "no explicit flush: one step streams several GB of activations, far beyond the 126 MB L2",
+                   "l2": "no explicit flush: one step streams several GB of activations, far beyond the 50 MB L2",
                    "kernel_impl": ops.get_impl(), "spatial_reorder": not args.no_reorder, "loss_last": main.get("loss_last"),
                    "binding": "compiled" if ops.binding() is not None else "ctypes"},
         "e2e": {"value": main.get("e2e_value"), "unit": UNIT, "h2d_bytes_per_step": main["h2d_bytes"], "d2h_bytes_per_step": 4},

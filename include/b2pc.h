@@ -1,5 +1,5 @@
 /*
- * b2pc.h -- C ABI of libb2pc.so, the B200 (sm_100a) point-cloud backbone operator library.
+ * b2pc.h -- C ABI of libb2pc.so, the H100 (sm_90a) point-cloud backbone operator library.
  *
  * This is the drop-in boundary for the two third-party operator packages Pointcept's
  * PT-v3m1 / SpUNet-v1m1 hot path calls (the reference itself has no C ABI: its in-repo
@@ -81,8 +81,8 @@ int b2pc_patch_padding(const int64_t* offset, int batch_size, int patch_size, in
  * point_transformer_v3m1_base.py:208-214 (non-causal, no dropout, no mask).
  * qkv [T,3,H,D] contiguous (fp16 or bf16), cu_seqlens [n_seq+1] int32, out [T,H,D] (same dtype),
  * lse [H,T] fp32 (natural-log sum-exp of scale*QK^T, flash-attn's softmax_lse layout).
- * impl: 0 = auto (tcgen05 kernel when the shape is supported), 1 = SIMT reference kernel,
- *       2 = tcgen05 kernel (error if unsupported).
+ * impl: 0 = auto (tensor-core kernel when the shape is supported), 1 = SIMT reference kernel,
+ *       2 = tensor-core kernel (error if unsupported).
  * ------------------------------------------------------------------------------------------- */
 int b2pc_patch_attn_fwd(const void* qkv, int dtype, const int32_t* cu_seqlens, int n_seq, int max_seqlen,
                         int64_t t, int heads, int head_dim, float scale, void* out, float* lse,

@@ -1,4 +1,4 @@
-"""pointcept_b200 -- B200 (sm_100a) operators behind Pointcept's PT-v3 / SpUNet hot path.
+"""pointcept_b200 -- H100 (sm_90a) operators behind Pointcept's PT-v3 / SpUNet hot path.
 
 ``install()`` registers the drop-in modules under the import names the reference uses
 (``spconv``, ``spconv.pytorch``, optionally ``flash_attn``, and with ``extras=True`` ``pointrope`` and ``pointops.knn_query``) so unmodified Pointcept model files

@@ -8,7 +8,7 @@ import sys
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2pc.so")
 CSRC = os.path.join(_HERE, "csrc")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-Xlinker", "-soname=libb2pc.so"]
 BINDING_DIR = os.path.join(_HERE, "_build_torch_binding")
 BINDING_PATH = os.path.join(BINDING_DIR, "_b2pc_torch.so")
@@ -139,10 +139,8 @@ EXPORTS = tuple(_SIGS)
 
 
 def build(verbose=False, extra_flags=()):
-    """Compile libb2pc.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile libb2pc.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     extra_flags = list(extra_flags)
-    if not os.path.exists(os.path.join(CSRC, "attn_umma.cuh")) and "-DB2PC_NO_UMMA" not in extra_flags:
-        extra_flags.append("-DB2PC_NO_UMMA")
     cmd = ["nvcc"] + NVCC_FLAGS + extra_flags + [os.path.join(CSRC, "b2pc.cu"), "-o", LIB_PATH]
     if verbose:
         print(" ".join(cmd), file=sys.stderr)
@@ -195,7 +193,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"pointcept_b200: {LIB_PATH} not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU or PyTorch fallback for these operators.")
+                "(nvcc, sm_90a). There is no CPU or PyTorch fallback for these operators.")
         l = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL)
         for name, (res, args) in _SIGS.items():
             fn = getattr(l, name)  # raises AttributeError if the symbol is missing

@@ -1,5 +1,5 @@
 // SIMT patch attention (one thread per query / per key, fp32 math): the always-available correctness
-// path and the on-GPU A/B reference for the tcgen05 kernels in attn_umma.cuh.
+// path and the on-GPU A/B reference for the tensor-core kernels in attn_mma.cuh.
 // Layouts follow flash_attn_varlen_qkvpacked_func: qkv [T,3,H,D], out [T,H,D], lse [H,T] (natural log).
 #pragma once
 #include "common.cuh"

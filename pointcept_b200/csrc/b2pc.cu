@@ -1,4 +1,4 @@
-// libb2pc.so -- C ABI (include/b2pc.h) over the sm_100a kernels.  No torch types cross this boundary.
+// libb2pc.so -- C ABI (include/b2pc.h) over the sm_90a kernels.  No torch types cross this boundary.
 #include <stdarg.h>
 
 #include "common.cuh"
@@ -13,11 +13,8 @@
 #include "voxelize.cuh"
 #include "eval_ops.cuh"
 #include "loss.cuh"
-#ifndef B2PC_NO_UMMA
-#include "attn_umma.cuh"
-#include "spconv_umma.cuh"
-#include "spconv_ws.cuh"
-#endif
+#include "attn_mma.cuh"
+#include "spconv_mma.cuh"
 
 #include <atomic>
 #include <mutex>
@@ -60,19 +57,6 @@ struct ProfScope {
 }  // namespace
 #define B2PC_PROF(stream, id, flops, bytes) ProfScope prof_scope__((stream), (id), (double)(flops), (double)(bytes))
 
-// Sparse-conv kernel generations (A/B switches).  Weight gradient: the warp-specialised persistent kernel (wgrad_ws_kernel) is the
-// default, B2PC_CONV_V1=1 selects the round-1 kernel.  Forward / backward-data: the round-1 output-stationary kernel
-// (gather_gemm_umma_kernel, 4 CTAs per SM) is still the faster one on B200 (profiles/README.md) and stays the default;
-// B2PC_CONV_WS=1 selects the warp-specialised conv_ws_kernel.
-static bool conv_v1() {
-  static const bool v = [] { const char* e = getenv("B2PC_CONV_V1"); return e && atoi(e) != 0; }();
-  return v;
-}
-static bool conv_fwd_ws() {
-  static const bool v = [] { const char* e = getenv("B2PC_CONV_WS"); return e && atoi(e) != 0; }();
-  return v && !conv_v1();
-}
-
 extern "C" {
 
 int b2pc_version(void) { return 100; }
@@ -110,24 +94,18 @@ int b2pc_patch_attn_fwd(const void* qkv, int dtype, const int32_t* cu_seqlens, i
   B2PC_CHECK_ARG(dtype == B2PC_F16 || dtype == B2PC_BF16, "patch_attn_fwd: dtype must be fp16 or bf16 (got %d)", dtype);
   B2PC_CHECK_ARG(n_seq >= 0 && max_seqlen >= 0 && t >= 0 && heads > 0 && head_dim > 0, "patch_attn_fwd: bad sizes");
   cudaStream_t s = (cudaStream_t)stream;
-#ifndef B2PC_NO_UMMA
   if (impl != 1) {
-    if (attn_umma_supported(dtype, head_dim)) return launch_attn_fwd_umma(qkv, dtype, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, out, lse, s);
-    if (impl == 2) { set_error("patch_attn_fwd: tcgen05 kernel does not support dtype %d head_dim %d", dtype, head_dim); return B2PC_ERR_UNSUPPORTED; }
+    if (attn_mma_supported(dtype, head_dim)) return launch_attn_fwd_mma(qkv, dtype, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, out, lse, s);
+    if (impl == 2) { set_error("patch_attn_fwd: tensor-core kernel does not support dtype %d head_dim %d", dtype, head_dim); return B2PC_ERR_UNSUPPORTED; }
   }
-#else
-  if (impl == 2) { set_error("patch_attn_fwd: built without tcgen05 kernels"); return B2PC_ERR_UNSUPPORTED; }
-#endif
   if (dtype == B2PC_F16) return launch_attn_fwd_simt<__half>(qkv, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, out, lse, s);
   return launch_attn_fwd_simt<__nv_bfloat16>(qkv, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, out, lse, s);
 }
 
 size_t b2pc_patch_attn_bwd_workspace_bytes(int64_t t, int heads, int head_dim) {
   size_t b = attn_bwd_workspace_bytes(t, heads, head_dim);
-#ifndef B2PC_NO_UMMA
-  size_t u = attn_bwd_umma_workspace_bytes(t, heads, head_dim);
+  size_t u = attn_bwd_mma_workspace_bytes(t, heads, head_dim);
   if (u > b) b = u;
-#endif
   return b;
 }
 
@@ -139,14 +117,10 @@ int b2pc_patch_attn_bwd(const void* dout, const void* qkv, const void* out, cons
   B2PC_CHECK_ARG(dtype == B2PC_F16 || dtype == B2PC_BF16, "patch_attn_bwd: dtype must be fp16 or bf16 (got %d)", dtype);
   if (workspace_bytes < b2pc_patch_attn_bwd_workspace_bytes(t, heads, head_dim)) { set_error("patch_attn_bwd: workspace too small"); return B2PC_ERR_WORKSPACE; }
   cudaStream_t s = (cudaStream_t)stream;
-#ifndef B2PC_NO_UMMA
   if (impl != 1) {
-    if (attn_umma_supported(dtype, head_dim)) return launch_attn_bwd_umma(dout, qkv, out, lse, dtype, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, dqkv, workspace, s);
-    if (impl == 2) { set_error("patch_attn_bwd: tcgen05 kernel does not support dtype %d head_dim %d", dtype, head_dim); return B2PC_ERR_UNSUPPORTED; }
+    if (attn_mma_supported(dtype, head_dim)) return launch_attn_bwd_mma(dout, qkv, out, lse, dtype, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, dqkv, workspace, s);
+    if (impl == 2) { set_error("patch_attn_bwd: tensor-core kernel does not support dtype %d head_dim %d", dtype, head_dim); return B2PC_ERR_UNSUPPORTED; }
   }
-#else
-  if (impl == 2) { set_error("patch_attn_bwd: built without tcgen05 kernels"); return B2PC_ERR_UNSUPPORTED; }
-#endif
   if (dtype == B2PC_F16) return launch_attn_bwd_simt<__half>(dout, qkv, out, lse, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, dqkv, workspace, s);
   return launch_attn_bwd_simt<__nv_bfloat16>(dout, qkv, out, lse, cu_seqlens, n_seq, max_seqlen, t, heads, head_dim, scale, dqkv, workspace, s);
 }
@@ -184,12 +158,7 @@ int b2pc_rulebook_strided_finish(const int32_t* indices, int64_t n, const int* s
 
 // ---- sparse convolution arithmetic ---------------------------------------------------------------------
 size_t b2pc_spconv_gather_gemm_workspace_bytes(int64_t n_out, int c_in, int c_out, int kv) {
-#ifndef B2PC_NO_UMMA
-  if (conv_fwd_ws()) return 0;
-  return conv_umma_workspace_bytes(n_out, c_in, c_out, kv);
-#else
-  return 0;
-#endif
+  return conv_mma_workspace_bytes(n_out, c_in, c_out, kv);
 }
 
 int b2pc_spconv_gather_gemm(const void* feat, const void* weight, const void* bias, const int32_t* pair, int64_t pair_stride,
@@ -200,20 +169,14 @@ int b2pc_spconv_gather_gemm(const void* feat, const void* weight, const void* bi
   B2PC_CHECK_ARG(feat && weight && pair && out, "spconv_gather_gemm: null pointer");
   B2PC_CHECK_ARG(n_in >= 0 && n_out >= 0 && c_in > 0 && c_out > 0 && kv > 0 && pair_stride >= n_out, "spconv_gather_gemm: bad sizes");
   cudaStream_t s = (cudaStream_t)stream;
-#ifndef B2PC_NO_UMMA
   if (impl != 1) {
-    if (conv_fwd_ws() && conv_ws_supported(dtype, c_in, c_out, kv))
-      return launch_conv_ws(feat, weight, bias, pair, pair_stride, n_out, c_in, c_out, kv, transpose_w, flip, dtype, out, s);
-    if (spconv_umma_supported(dtype, c_in, c_out)) {
-      const size_t need = conv_umma_workspace_bytes(n_out, c_in, c_out, kv);
-      if (need > 0 && (!workspace || workspace_bytes < need)) { set_error("spconv_gather_gemm: workspace too small"); return B2PC_ERR_WORKSPACE; }
-      return launch_gather_gemm_umma(feat, weight, bias, pair, pair_stride, n_in, n_out, c_in, c_out, kv, transpose_w, flip, dtype, out, workspace, s);
+    if (spconv_mma_supported(dtype, c_in, c_out)) {
+      const size_t need = conv_mma_workspace_bytes(n_out, c_in, c_out, kv);
+      if (!workspace || workspace_bytes < need) { set_error("spconv_gather_gemm: workspace too small"); return B2PC_ERR_WORKSPACE; }
+      return launch_gather_gemm_mma(feat, weight, bias, pair, pair_stride, n_out, c_in, c_out, kv, transpose_w, flip, dtype, out, workspace, s);
     }
-    if (impl == 2) { set_error("spconv_gather_gemm: tcgen05 kernel does not support dtype %d c_in %d c_out %d", dtype, c_in, c_out); return B2PC_ERR_UNSUPPORTED; }
+    if (impl == 2) { set_error("spconv_gather_gemm: tensor-core kernel does not support dtype %d c_in %d c_out %d", dtype, c_in, c_out); return B2PC_ERR_UNSUPPORTED; }
   }
-#else
-  if (impl == 2) { set_error("spconv_gather_gemm: built without tcgen05 kernels"); return B2PC_ERR_UNSUPPORTED; }
-#endif
   switch (dtype) {
     case B2PC_F32: return launch_gather_gemm_simt<float>(feat, weight, bias, pair, pair_stride, n_out, c_in, c_out, kv, transpose_w, flip, out, s);
     case B2PC_F16: return launch_gather_gemm_simt<__half>(feat, weight, bias, pair, pair_stride, n_out, c_in, c_out, kv, transpose_w, flip, out, s);
@@ -225,12 +188,8 @@ int b2pc_spconv_gather_gemm(const void* feat, const void* weight, const void* bi
 
 size_t b2pc_spconv_bwd_weight_workspace_bytes(int64_t n_out, int c_in, int c_out, int kv) {
   size_t b = bwd_weight_workspace_bytes(n_out, c_in, c_out, kv);
-#ifndef B2PC_NO_UMMA
-  size_t u = wgrad_umma_workspace_bytes(n_out, c_in, c_out, kv);
+  size_t u = wgrad_mma_workspace_bytes(n_out, c_in, c_out, kv);
   if (u > b) b = u;
-  u = wgrad_ws_workspace_bytes(n_out, c_in, c_out, kv);
-  if (u > b) b = u;
-#endif
   return b;
 }
 
@@ -243,16 +202,10 @@ int b2pc_spconv_bwd_weight(const void* feat_in, const void* dout, const int32_t*
   B2PC_CHECK_ARG(n_in >= 0 && n_out >= 0 && c_in > 0 && c_out > 0 && kv > 0 && pair_stride >= n_out, "spconv_bwd_weight: bad sizes");
   cudaStream_t s = (cudaStream_t)stream;
   if (workspace_bytes < b2pc_spconv_bwd_weight_workspace_bytes(n_out, c_in, c_out, kv)) { set_error("spconv_bwd_weight: workspace too small"); return B2PC_ERR_WORKSPACE; }
-#ifndef B2PC_NO_UMMA
   if (impl != 1 && n_out > 0) {
-    if (!conv_v1() && wgrad_ws_supported(dtype, c_in, c_out, kv))
-      return launch_wgrad_ws(feat_in, dout, pair, pair_stride, n_out, c_in, c_out, kv, dtype, dweight, workspace, s);
-    if (wgrad_umma_supported(dtype, c_in, c_out)) return launch_bwd_weight_umma(feat_in, dout, pair, pair_stride, n_out, c_in, c_out, kv, dtype, dweight, workspace, s);
-    if (impl == 2) { set_error("spconv_bwd_weight: tcgen05 kernel does not support dtype %d c_in %d c_out %d", dtype, c_in, c_out); return B2PC_ERR_UNSUPPORTED; }
+    if (wgrad_mma_supported(dtype, c_in, c_out)) return launch_bwd_weight_mma(feat_in, dout, pair, pair_stride, n_out, c_in, c_out, kv, dtype, dweight, workspace, s);
+    if (impl == 2) { set_error("spconv_bwd_weight: tensor-core kernel does not support dtype %d c_in %d c_out %d", dtype, c_in, c_out); return B2PC_ERR_UNSUPPORTED; }
   }
-#else
-  if (impl == 2) { set_error("spconv_bwd_weight: built without tcgen05 kernels"); return B2PC_ERR_UNSUPPORTED; }
-#endif
   switch (dtype) {
     case B2PC_F32: return launch_bwd_weight_simt<float>(feat_in, dout, pair, pair_stride, n_out, c_in, c_out, kv, dweight, workspace, workspace_bytes, s);
     case B2PC_F16: return launch_bwd_weight_simt<__half>(feat_in, dout, pair, pair_stride, n_out, c_in, c_out, kv, dweight, workspace, workspace_bytes, s);
@@ -338,21 +291,15 @@ int b2pc_serialized_attn_fwd(const void* qkv_points, int dtype, const int32_t* g
   B2PC_PROF(stream, B2PC_P_ATTN_FWD, 4.0 * t_pad * max_seqlen * heads * head_dim, 16.0 * t_pad * heads * head_dim);
   B2PC_CHECK_ARG(qkv_points && gidx && sidx && cu_seqlens && out_points && lse, "serialized_attn_fwd: null pointer");
   B2PC_CHECK_ARG(n_seq >= 0 && max_seqlen >= 0 && t_pad >= 0 && heads > 0 && head_dim > 0, "serialized_attn_fwd: bad sizes");
-#ifndef B2PC_NO_UMMA
-  if (attn_umma_supported(dtype, head_dim))
-    return launch_attn_fwd_umma(qkv_points, dtype, cu_seqlens, n_seq, max_seqlen, t_pad, heads, head_dim, scale, out_points, lse,
-                                (cudaStream_t)stream, gidx, sidx);
-#endif
-  set_error("serialized_attn_fwd: needs the tcgen05 kernel (fp16/bf16, head_dim 16); got dtype %d head_dim %d", dtype, head_dim);
+  if (attn_mma_supported(dtype, head_dim))
+    return launch_attn_fwd_mma(qkv_points, dtype, cu_seqlens, n_seq, max_seqlen, t_pad, heads, head_dim, scale, out_points, lse,
+                               (cudaStream_t)stream, gidx, sidx);
+  set_error("serialized_attn_fwd: needs the tensor-core kernel (fp16/bf16, head_dim 16); got dtype %d head_dim %d", dtype, head_dim);
   return B2PC_ERR_UNSUPPORTED;
 }
 
 size_t b2pc_serialized_attn_bwd_workspace_bytes(int64_t t_pad, int heads, int head_dim, int64_t n_dup) {
-#ifndef B2PC_NO_UMMA
-  return attn_bwd_umma_workspace_bytes(t_pad, heads, head_dim, n_dup);
-#else
-  return 0;
-#endif
+  return attn_bwd_mma_workspace_bytes(t_pad, heads, head_dim, n_dup);
 }
 
 int b2pc_serialized_attn_bwd(const void* dout_points, const void* qkv_points, const void* out_points, const float* lse, int dtype,
@@ -363,14 +310,12 @@ int b2pc_serialized_attn_bwd(const void* dout_points, const void* qkv_points, co
   B2PC_CHECK_ARG(dout_points && qkv_points && out_points && lse && gidx && sidx && cu_seqlens && dqkv_points && workspace,
                  "serialized_attn_bwd: null pointer");
   B2PC_CHECK_ARG(n_dup == 0 || dup_point, "serialized_attn_bwd: dup_point missing");
-#ifndef B2PC_NO_UMMA
-  if (attn_umma_supported(dtype, head_dim)) {
-    if (workspace_bytes < attn_bwd_umma_workspace_bytes(t_pad, heads, head_dim, n_dup)) { set_error("serialized_attn_bwd: workspace too small"); return B2PC_ERR_WORKSPACE; }
-    return launch_attn_bwd_umma(dout_points, qkv_points, out_points, lse, dtype, cu_seqlens, n_seq, max_seqlen, t_pad, heads, head_dim, scale,
-                                dqkv_points, workspace, (cudaStream_t)stream, gidx, sidx, dup_point, n_dup);
+  if (attn_mma_supported(dtype, head_dim)) {
+    if (workspace_bytes < attn_bwd_mma_workspace_bytes(t_pad, heads, head_dim, n_dup)) { set_error("serialized_attn_bwd: workspace too small"); return B2PC_ERR_WORKSPACE; }
+    return launch_attn_bwd_mma(dout_points, qkv_points, out_points, lse, dtype, cu_seqlens, n_seq, max_seqlen, t_pad, heads, head_dim, scale,
+                               dqkv_points, workspace, (cudaStream_t)stream, gidx, sidx, dup_point, n_dup);
   }
-#endif
-  set_error("serialized_attn_bwd: needs the tcgen05 kernel (fp16/bf16, head_dim 16); got dtype %d head_dim %d", dtype, head_dim);
+  set_error("serialized_attn_bwd: needs the tensor-core kernel (fp16/bf16, head_dim 16); got dtype %d head_dim %d", dtype, head_dim);
   return B2PC_ERR_UNSUPPORTED;
 }
 

@@ -1,4 +1,4 @@
-// Shared helpers for libb2pc (sm_100a only).
+// Shared helpers for libb2pc (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -10,7 +10,7 @@
 
 namespace b2pc {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 void set_error(const char* fmt, ...);
 void count_launches(int n);  // kernels launched by this library (b2pc_launch_count)

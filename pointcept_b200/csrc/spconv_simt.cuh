@@ -1,5 +1,5 @@
 // SIMT (CUDA-core, fp32 accumulate) sparse-convolution kernels: the always-available correctness path
-// and the on-GPU A/B reference for the tcgen05 kernels in spconv_umma.cuh.
+// and the on-GPU A/B reference for the tensor-core kernels in spconv_mma.cuh.
 #pragma once
 #include "common.cuh"
 

@@ -12,7 +12,7 @@ from . import _lib
 ORDER_IDS = {"z": 0, "z-trans": 1, "hilbert": 2, "hilbert-trans": 3}
 _DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
-# 0 = auto (tcgen05 kernels where supported), 1 = SIMT reference kernels, 2 = tcgen05 or error
+# 0 = auto (tensor-core kernels where supported), 1 = SIMT reference kernels, 2 = tensor-core kernels or error
 _impl = int(os.environ.get("B2PC_IMPL", "0"))
 
 

@@ -1,4 +1,4 @@
-"""PT-v3m1 backbone on the B200 operators: host-side mirror of
+"""PT-v3m1 backbone on the CUDA operators: host-side mirror of
 pointcept/models/point_transformer_v3/point_transformer_v3m1_base.py (module tree, parameter names and
 shapes identical, so reference checkpoints load), used as the workload of bench.py and the parity tests.
 
@@ -235,7 +235,7 @@ class SerializedAttention(PointModule):
             point[key] = (order_pad, primary_pos, dup_slots, order_pad[dup_slots])
         return point[key]
 
-    # class switch: gather-fused serialized attention (one operator) when the compiled binding + tcgen05 path apply
+    # class switch: gather-fused serialized attention (one operator) when the compiled binding + tensor-core path apply
     fused = os.environ.get("B2PC_ATTN_FUSED", "1") != "0"
 
     @torch.no_grad()

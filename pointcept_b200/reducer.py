@@ -2,12 +2,12 @@
 
 The reference wraps the model in ``DistributedDataParallel`` (pointcept/engines/defaults.py:22-43, one process per GPU from
 pointcept/engines/launch.py:73): an autograd hook per parameter (486 for PT-v3m1 base) copies each gradient into a bucket and
-launches the bucket's all-reduce.  On a B200 the training step is a ~29 ms chain of ~1 600 launches that the host barely keeps
+launches the bucket's all-reduce.  The training step is a chain of well over a thousand short launches that the host has to keep
 ahead of; 486 hook calls per step are then paid in wall time, not hidden.  ``FlatGradReducer`` does the same exchange (average
 of every gradient over the ranks, fp32, in place) with ONE autograd hook and at most two collectives per step:
 
 * all gradients are packed into one flat fp32 buffer by one launch of ``b2pc_multi_cast`` (fp32 -> fp32: a multi-tensor copy,
-  ~0.1 ms for 185 MB), laid out in the order the backward pass produces them (measured on the first step, agreed across ranks);
+  185 MB), laid out in the order the backward pass produces them (measured on the first step, agreed across ranks);
 * when the gradient of the *trigger* parameter arrives -- the point of the backward pass at which ``early_fraction`` of the
   gradient bytes exist (for PT-v3 that is inside encoder stage 3: the wide, cheap stages are behind, the narrow full-resolution
   stages that take most of the time are still ahead) -- the prefix of the buffer is packed and its all-reduce starts on NCCL's
@@ -15,7 +15,7 @@ of every gradient over the ranks, fp32, in place) with ONE autograd hook and at 
 * ``finish()`` packs and reduces the small remainder, waits for the early collective and points every ``p.grad`` at its slice of
   the flat buffer, where the (fused) optimizer reads it.
 
-NVLink 5 / NVSwitch moves the whole 185 MB in well under a millisecond, so two large messages beat many small buckets: the
+NVLink / NVSwitch moves the whole 185 MB in about a millisecond, so two large messages beat many small buckets: the
 exchange is sized for launch latency and overlap, not for link count.  No activation, rulebook or sort ever crosses GPUs.
 
 The pack is CUDA only (no CPU fallback); the CPU tests inject a packer to exercise the protocol under gloo.

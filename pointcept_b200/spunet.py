@@ -1,4 +1,4 @@
-"""SpUNet-v1m1 on the B200 sparse-conv operators: host-side mirror of
+"""SpUNet-v1m1 on the CUDA sparse-conv operators: host-side mirror of
 pointcept/models/sparse_unet/spconv_unet_v1m1_base.py:23-280 (same module tree / parameter names)."""
 from collections import OrderedDict
 from functools import partial

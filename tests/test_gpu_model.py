@@ -9,6 +9,7 @@ import torch
 
 from oracle import ptv3_cpu
 from oracle import spunet_cpu
+from oracle import fixture_dout, fixture_state_dict
 from oracle import spconv_ref as osp
 from pointcept_b200 import ops, synth
 from pointcept_b200.ptv3 import PointTransformerV3
@@ -35,7 +36,7 @@ def _tiny_model(sd):
 @pytest.mark.parametrize("impl", [1, 0])
 def test_ptv3_tiny_matches_reference_model(golden_dir, impl):
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     model = _tiny_model(sd)
     data = dict(coord=torch.from_numpy(g["coord"]).to(DEV), grid_coord=torch.from_numpy(g["grid_coord"]).to(DEV),
                 feat=torch.from_numpy(g["feat"]).to(DEV), offset=torch.from_numpy(g["offset"]).to(DEV))
@@ -43,7 +44,7 @@ def test_ptv3_tiny_matches_reference_model(golden_dir, impl):
     ops.set_impl(impl)
     try:
         out = model(data).feat
-        out.backward(torch.from_numpy(g["dout"]).to(DEV))
+        out.backward(fixture_dout(g).to(DEV))
     finally:
         ops.set_impl(old)
     # fp32 everywhere except the attention core, which takes bf16 q/k/v and returns bf16 (reference :209,:215):
@@ -58,7 +59,7 @@ def test_ptv3_tiny_matches_reference_model(golden_dir, impl):
 def test_ptv3_tiny_vs_cpu_oracle_with_bf16_attention_emulated(golden_dir):
     """Same rounding points on both sides (bf16 at the attention boundary): tighter tolerance, fresh input."""
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     model = _tiny_model(sd)
     b = synth.make_batch(3, seed=21, target_voxels=900)
     data = dict(coord=torch.from_numpy(b["coord"]).to(DEV), grid_coord=torch.from_numpy(b["grid_coord"]).to(DEV),
@@ -74,7 +75,7 @@ def test_ptv3_tiny_backward_all_parameter_gradients_vs_cpu_oracle(golden_dir):
     the same bf16 rounding points at the attention boundary (ptv3m1:209,215).  <= 1e-2 relative per parameter; a dropped
     borrowed-token gradient or a wrong offset flip in the conv backward shows up as O(1)."""
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     model = _tiny_model(sd)
     b = synth.make_batch(3, seed=22, target_voxels=1100)     # 3 scenes: padded + borrowed patches at every level
     data = dict(coord=torch.from_numpy(b["coord"]).to(DEV), grid_coord=torch.from_numpy(b["grid_coord"]).to(DEV),
@@ -112,10 +113,10 @@ def test_ptv3_tiny_backward_all_parameter_gradients_vs_cpu_oracle(golden_dir):
 @pytest.mark.parametrize("amp", [torch.bfloat16, torch.float16])
 def test_ptv3_tiny_autocast_runs_tensor_core_convs_and_matches_oracle(golden_dir, amp):
     """Autocast step (stock configs run fp16 AMP + GradScaler: configs/_base_/default_runtime.py:19, engines/train.py:203,351):
-    features reach the sparse convs in half precision, so the tcgen05 conv kernels are on the path (B2PC_IMPL=2 semantics are
+    features reach the sparse convs in half precision, so the tensor-core conv kernels are on the path (B2PC_IMPL=2 semantics are
     asserted through the launch counter of the tensor-core entry points)."""
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     model = _tiny_model(sd)
     data = dict(coord=torch.from_numpy(g["coord"]).to(DEV), grid_coord=torch.from_numpy(g["grid_coord"]).to(DEV),
                 feat=torch.from_numpy(g["feat"]).to(DEV), offset=torch.from_numpy(g["offset"]).to(DEV))
@@ -128,7 +129,7 @@ def test_ptv3_tiny_autocast_runs_tensor_core_convs_and_matches_oracle(golden_dir
             opt.zero_grad(set_to_none=True)   # is skipped and the scale halves; the first step that fits is the one compared
             with torch.autocast("cuda", dtype=amp):
                 out = model(dict(data)).feat
-            loss = (out.float() * torch.from_numpy(g["dout"]).to(DEV)).sum()
+            loss = (out.float() * fixture_dout(g).to(DEV)).sum()
             scale_before = scaler.get_scale()
             scaler.scale(loss).backward()
             scaler.unscale_(opt)
@@ -154,7 +155,7 @@ def test_ptv3_tiny_autocast_runs_tensor_core_convs_and_matches_oracle(golden_dir
 
 def test_spatial_reorder_is_permutation_equivalent(golden_dir):
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     data = dict(coord=torch.from_numpy(g["coord"]).to(DEV), grid_coord=torch.from_numpy(g["grid_coord"]).to(DEV),
                 feat=torch.from_numpy(g["feat"]).to(DEV), offset=torch.from_numpy(g["offset"]).to(DEV))
     outs = []
@@ -317,7 +318,7 @@ def test_compiled_binding_matches_ctypes_binding(golden_dir):
     assert torch.equal(a[0], b_[0]) and rel_l2(b_[1], a[1]) < 1e-2
 
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     data = dict(coord=torch.from_numpy(g["coord"]).to(DEV), grid_coord=torch.from_numpy(g["grid_coord"]).to(DEV),
                 feat=torch.from_numpy(g["feat"]).to(DEV), offset=torch.from_numpy(g["offset"]).to(DEV))
 
@@ -358,10 +359,10 @@ def test_flat_grad_reducer_nccl_packs_bit_exact_and_feeds_fused_adamw(golden_dir
     from pointcept_b200.optim import FusedAdamW
     from pointcept_b200.reducer import FlatGradReducer
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     data = dict(coord=torch.from_numpy(g["coord"]).to(DEV), grid_coord=torch.from_numpy(g["grid_coord"]).to(DEV),
                 feat=torch.from_numpy(g["feat"]).to(DEV), offset=torch.from_numpy(g["offset"]).to(DEV))
-    dout = torch.from_numpy(g["dout"]).to(DEV)
+    dout = fixture_dout(g).to(DEV)
     own_pg = not dist.is_initialized()
     if own_pg:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")

@@ -270,7 +270,7 @@ def test_patch_attention_matches_reference_dense_branch_fixture(golden_dir):
 
 
 def test_patch_attention_against_flash_attn_if_present():
-    """On the B200 box flash-attn 2.8.3 (the package the reference pins, scripts/build_image.sh:73) is the GPU oracle."""
+    """Where it is installed, flash-attn 2.8.3 (the package the reference pins, scripts/build_image.sh:73) is the GPU oracle."""
     fa = pytest.importorskip("flash_attn")
     if not hasattr(fa, "flash_attn_varlen_qkvpacked_func") or "b2pc" in getattr(fa, "__version__", ""):
         pytest.skip("stock flash_attn not importable")
@@ -293,7 +293,7 @@ def test_patch_attention_against_flash_attn_if_present():
     assert rel_l2(qkv.grad.float(), gref.float()) < 8e-3
 
 
-# ---- tcgen05 kernels (impl=2): same oracles, plus A/B against the SIMT kernels at full size ---------------------------
+# ---- tensor-core kernels (impl=2): same oracles, plus A/B against the SIMT kernels at full size ---------------------------
 @pytest.mark.parametrize("lens,H", [([1024], 2), ([1024, 1024, 1024], 4), ([48, 48, 48], 2), ([700], 2), ([1024, 333, 1, 129, 128], 3),
                                     ([2048, 100], 1)])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -301,6 +301,27 @@ def test_patch_attention_tcgen05_vs_oracle(lens, H, dtype):
     # P is rounded to the MMA operand type (bf16: 8 bits) before PV: 3e-3 on the output for bf16, 1e-3 for fp16
     _attn_case(lens, H, 16, dtype, impl=2, tol_out=3e-3 if dtype == torch.bfloat16 else 1e-3,
                tol_grad=6e-3 if dtype == torch.bfloat16 else 2e-3)
+
+
+def test_tensor_core_attention_gradients_are_bitwise_reproducible():
+    """Same inputs, same bits: the backward forms every gradient element in a fixed order (no atomics), so two calls agree exactly."""
+    torch.manual_seed(0)
+    lens = [1024] * 6 + [333]
+    T, H = sum(lens), 2
+    cu = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int32, device=DEV)
+    qkv = (torch.randn(T, 3, H, 16, device=DEV) * 1.5).bfloat16()
+    dout = torch.randn(T, H, 16, device=DEV).bfloat16()
+    grads = []
+    old = ops.get_impl()
+    ops.set_impl(2)
+    try:
+        for _ in range(2):
+            q = qkv.clone().requires_grad_(True)
+            ops.patch_attention(q, cu, 1024, 0.25).backward(dout)
+            grads.append(q.grad)
+    finally:
+        ops.set_impl(old)
+    assert torch.equal(grads[0], grads[1])
 
 
 @pytest.mark.parametrize("cin,cout", [(32, 32), (64, 64), (96, 96), (128, 64), (16, 48), (256, 256), (384, 256), (512, 512)])

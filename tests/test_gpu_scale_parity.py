@@ -38,7 +38,7 @@ def _pair(ks):
     return s["pairs"][ks]
 
 
-# ---- sparse convolution: tcgen05 kernels vs the oracle on one full scene (SubM call sites of ptv3m1:278-284,499-506 and
+# ---- sparse convolution: tensor-core kernels vs the oracle on one full scene (SubM call sites of ptv3m1:278-284,499-506 and
 # spunet:43-68,114-121; 128->96 is SpUNet's dec0 width) ------------------------------------------------------------------
 @pytest.mark.parametrize("cin,cout,ks", [(32, 32, 3), (64, 64, 3), (16, 32, 5), (128, 96, 3)])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
@@ -62,7 +62,7 @@ def test_tcgen05_conv_vs_oracle_full_scene(cin, cout, ks, dtype):
     ref.backward(dout.double())
     fg, wg, bg = feat.to(DEV).requires_grad_(True), w.float().to(DEV).requires_grad_(True), b.float().to(DEV).requires_grad_(True)
     old = ops.get_impl()
-    ops.set_impl(2)     # tcgen05 or error: a silent SIMT fallback cannot pass for the tensor-core path
+    ops.set_impl(2)     # tensor cores or error: a silent SIMT fallback cannot pass for the tensor-core path
     try:
         out = ops.sparse_conv(fg, wg, bg, pair, pair, True)
         out.backward(dout.to(DEV))

@@ -10,7 +10,6 @@ import pytest
 import torch
 
 from pointcept_b200 import synth
-from tools import ref_import
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -47,30 +46,29 @@ def test_dropin_modules_register_under_reference_import_names():
         del sys.modules[k]
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="/root/reference only exists in the authoring container")
-def test_unmodified_reference_models_build_on_the_dropins_with_identical_state_dict():
-    """The reference's own PT-v3m1 / SpUNet-v1m1 files, imported unmodified on top of our spconv / flash_attn
-    modules, produce the same parameter names and shapes as the mirrors (checkpoint ABI)."""
+def test_unmodified_reference_models_build_on_the_dropins_with_identical_state_dict(golden_dir):
+    """The reference's own PT-v3m1 / SpUNet-v1m1 files, imported unmodified on top of our spconv / flash_attn modules
+    (tests/golden/reference_dropin.npz, tools/gen_golden.py::gen_dropin_abi), produce the same parameter names and shapes as the
+    mirrors (checkpoint ABI), and the reference's Point.sparsify() builds the same SparseConvTensor as the mirror's."""
     from pointcept_b200.ptv3 import PointTransformerV3, ptv3_base_config
     from pointcept_b200.spunet import SpUNetBase
-    ref = ref_import.load_models(use_shims=True)
-    a = {k: tuple(v.shape) for k, v in PointTransformerV3(**ptv3_base_config()).state_dict().items()}
-    b = {k: tuple(v.shape) for k, v in ref.ptv3.PointTransformerV3(**ptv3_base_config()).state_dict().items()}
-    assert a == b and len(a) > 400
-    a = {k: tuple(v.shape) for k, v in SpUNetBase(6, 20).state_dict().items()}
-    b = {k: tuple(v.shape) for k, v in ref.spunet.SpUNetBase(6, 20).state_dict().items()}
-    assert a == b and len(a) > 300
-    # the reference's own Point.sparsify() (structure.py:112-148) builds OUR SparseConvTensor, and its PointSequential
-    # (modules.py:84) recognises our conv modules through spconv.modules.is_spconv_module
+    from pointcept_b200.structure import Point
+    ref = json.loads(str(np.load(os.path.join(golden_dir, "reference_dropin.npz"))["json"]))
+    a = [[k, list(v.shape)] for k, v in PointTransformerV3(**ptv3_base_config()).state_dict().items()]
+    assert a == ref["ptv3_base"] and len(a) > 400
+    a = [[k, list(v.shape)] for k, v in SpUNetBase(6, 20).state_dict().items()]
+    assert a == ref["spunet_6_20"] and len(a) > 300
+    import pointcept_b200
+    pointcept_b200.install(flash_attn=True)
     import spconv.pytorch as spconv
-    pt = ref.structure.Point(grid_coord=torch.randint(0, 50, (100, 3)), feat=torch.randn(100, 6), offset=torch.tensor([60, 100]))
+    sp = ref["sparsify"]
+    pt = Point(grid_coord=torch.tensor(sp["grid_coord"]), feat=torch.randn(len(sp["grid_coord"]), 6), offset=torch.tensor(sp["offset"]))
     pt.sparsify()
     x = pt.sparse_conv_feat
-    assert isinstance(x, spconv.SparseConvTensor) and x.indices.dtype == torch.int32 and x.batch_size == 2
-    assert x.spatial_shape == [int(v) + 96 for v in pt.grid_coord.max(0).values]
-    seq = ref.modules.PointSequential(spconv.SubMConv3d(6, 8, 3, indice_key="k"))
-    assert spconv.modules.is_spconv_module(seq[0])
-    for k in [k for k in sys.modules if k.split(".")[0] in ("spconv", "flash_attn", "pointcept", "addict", "timm", "torch_scatter", "torch_geometric")]:
+    assert isinstance(x, spconv.SparseConvTensor) and x.indices.dtype == torch.int32 and x.batch_size == sp["batch_size"]
+    assert x.indices.tolist() == sp["indices"] and [int(v) for v in x.spatial_shape] == sp["spatial_shape"]
+    assert spconv.modules.is_spconv_module(spconv.SubMConv3d(6, 8, 3, indice_key="k"))
+    for k in [k for k in sys.modules if k.split(".")[0] in ("spconv", "flash_attn")]:
         del sys.modules[k]
 
 
@@ -293,29 +291,8 @@ def test_non_flash_rpe_attention_branch_matches_reference_fixture(golden_dir):
     assert torch.allclose(attn.rpe.rpe_table.grad, torch.from_numpy(g["d_rpe_table"]), rtol=1e-4, atol=1e-6)
 
 
-def test_collate_fn_matches_the_reference_function():
-    """pointcept_b200.datasets.collate_fn vs the reference's own collate_fn (pointcept/datasets/utils.py:19-73) on CPU tensors: dicts with
-    per-sample offsets (what Collect emits), bare tensors, tuples of tensors (offset appended), lists of numbers, strings."""
-    if not ref_import.available():
-        pytest.skip("needs /root/reference")
-    import importlib.util
-    import types
-    from pointcept_b200 import datasets
-    saved = {k: sys.modules.get(k) for k in ("torch_scatter", "pointcept", "pointcept.models", "pointcept.models.utils")}
-    try:
-        sys.modules["torch_scatter"] = types.SimpleNamespace(scatter_min=None)
-        for name in ("pointcept", "pointcept.models"):
-            sys.modules[name] = types.ModuleType(name)
-        sys.modules["pointcept.models.utils"] = types.SimpleNamespace(offset2batch=None)
-        spec = importlib.util.spec_from_file_location("_ref_datasets_utils", os.path.join(ref_import.REF, "pointcept/datasets/utils.py"))
-        ref = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(ref)
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
+def collate_inputs():
+    """the seeded inputs of the collate_fn comparison (tools/gen_golden.py::gen_collate runs the reference on the same ones)"""
     g = torch.Generator().manual_seed(0)
 
     def sample(n, with_offset=True):
@@ -324,6 +301,19 @@ def test_collate_fn_matches_the_reference_function():
         if with_offset:
             d["offset"] = torch.tensor([n])
         return d
+
+    batch = [sample(5), sample(9), sample(1)]
+    tensors = [torch.randn(4, 2, generator=g), torch.randn(3, 2, generator=g)]
+    return dict(batch=batch, tensors=tensors, no_offset=[sample(5, False), sample(2, False)])
+
+
+def test_collate_fn_matches_the_reference_function(golden_dir):
+    """pointcept_b200.datasets.collate_fn vs the reference's own collate_fn (pointcept/datasets/utils.py:19-73) on CPU tensors: dicts with
+    per-sample offsets (what Collect emits), bare tensors, tuples of tensors (offset appended), lists of numbers, strings.  The
+    reference's results are stored in tests/golden/collate_fn.pt (tools/gen_golden.py::gen_collate)."""
+    from pointcept_b200 import datasets
+    ref = torch.load(os.path.join(golden_dir, "collate_fn.pt"), weights_only=True)
+    inp = collate_inputs()
 
     def same(a, b):
         if isinstance(a, torch.Tensor):
@@ -339,20 +329,17 @@ def test_collate_fn_matches_the_reference_function():
         else:
             assert a == b
 
-    batch = [sample(5), sample(9), sample(1)]
-    same(ref.collate_fn([dict(d) for d in batch]), datasets.collate_fn([dict(d) for d in batch]))
+    batch = inp["batch"]
+    same(ref["batch"], datasets.collate_fn([dict(d) for d in batch]))
     # a fragment list: per-sample offsets that already hold several scenes (test-time fragments are collated twice, test.py:170-176)
-    strip = lambda d: {k: v for k, v in d.items() if k != "name"}     # noqa: E731  (the reference cannot re-collate lists of str)
-    two = [ref.collate_fn([strip(d) for d in batch[:2]]), ref.collate_fn([strip(d) for d in batch[1:]])]
-    same(ref.collate_fn([dict(d) for d in two]), datasets.collate_fn([dict(d) for d in two]))
-    tensors = [torch.randn(4, 2, generator=g), torch.randn(3, 2, generator=g)]
-    same(ref.collate_fn(list(tensors)), datasets.collate_fn(list(tensors)))
+    same(ref["two"], datasets.collate_fn([dict(d) for d in ref["two_in"]]))
+    same(ref["tensors"], datasets.collate_fn(list(inp["tensors"])))
     # tuples of per-point tensors: the reference's Sequence branch (utils.py:35-40) appends to its samples, so it only serves
     # append-able non-list sequences; here tuples give the same result it describes: columns + cumulative int32 offset
     cols = datasets.collate_fn([(torch.ones(4, 3), torch.arange(4)), (torch.zeros(2, 3), torch.arange(2))])
     assert [tuple(c.shape) for c in cols] == [(6, 3), (6,), (2,)] and cols[2].tolist() == [4, 6] and cols[2].dtype == torch.int32
-    same(ref.collate_fn([[1, 2], [3]]), datasets.collate_fn([[1, 2], [3]]))
-    same(ref.collate_fn(["a", "b"]), datasets.collate_fn(["a", "b"]))
+    same(ref["numbers"], datasets.collate_fn([[1, 2], [3]]))
+    same(ref["strings"], datasets.collate_fn(["a", "b"]))
     # extension, documented: a dict without any offset key gets one from its coord lengths (the reference's datasets add it in Collect)
-    out = datasets.collate_fn([sample(5, False), sample(2, False)])
+    out = datasets.collate_fn(inp["no_offset"])
     assert out["offset"].tolist() == [5, 7]

@@ -5,12 +5,12 @@ import os
 import numpy as np
 import torch
 
-from oracle import ptv3_cpu
+from oracle import fixture_dout, fixture_state_dict, ptv3_cpu
 
 
 def _load(golden_dir):
     g = np.load(os.path.join(golden_dir, "ptv3_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     grads = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("grad::")}
     return g, sd, grads
 
@@ -26,7 +26,7 @@ def test_cpu_model_matches_reference_forward_backward(golden_dir):
     assert out.shape == ref.shape
     rel = (out.detach() - ref).norm() / ref.norm()
     assert rel < 1e-5, rel
-    out.backward(torch.from_numpy(g["dout"]))
+    out.backward(fixture_dout(g))
     for k, gr in grads.items():
         rel = (sd[k].grad - gr).norm() / gr.norm()
         assert rel < 1e-4, (k, rel)
@@ -38,7 +38,7 @@ def test_spunet_restatement_matches_unmodified_reference_model(golden_dir):
     import types
     from oracle import spunet_cpu
     g = np.load(os.path.join(golden_dir, "spunet_tiny.npz"))
-    sd = {k[4:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd::")}
+    sd = fixture_state_dict(g)
     grads = {k[6:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("grad::")}
     for v in sd.values():
         if v.is_floating_point():

@@ -168,6 +168,16 @@ def gen_attention_rpe():
 from oracle.ptv3_cpu import TINY_CFG  # noqa: E402
 
 
+def _seeded_weights(model, seed):
+    """load oracle.seeded_state_dict() into the reference model -> (the spec as a JSON string array, seed): the fixture stores
+    these instead of the weights themselves"""
+    import json
+    from oracle import seeded_state_dict
+    spec = [[k, list(v.shape)] for k, v in model.state_dict().items()]
+    model.load_state_dict(seeded_state_dict(spec, seed))
+    return np.array(json.dumps(spec)), np.int64(seed)
+
+
 def gen_ptv3_tiny():
     """The UNMODIFIED reference PT-v3m1 (non-flash fp32 attention branch) run on CPU, with spconv stood in by
     oracle/spconv_ref.py.  Pins the model-level restatement (blocks, pooling, unpooling quirk, padding)."""
@@ -182,6 +192,7 @@ def gen_ptv3_tiny():
     for m in model.modules():
         if hasattr(m, "shuffle_orders"):
             m.shuffle_orders = False
+    spec, seed = _seeded_weights(model, 3)
     scenes = [synth.indoor_scene(11, target_voxels=1400), synth.indoor_scene(12, target_voxels=1000)]
     grid = np.concatenate([s[1] for s in scenes])
     coord = np.concatenate([s[0] for s in scenes])
@@ -189,15 +200,15 @@ def gen_ptv3_tiny():
     feat = torch.randn(len(grid), 6)
     out = model(dict(coord=torch.from_numpy(coord), grid_coord=torch.from_numpy(grid), feat=feat,
                      offset=torch.from_numpy(offset)))
-    g = torch.randn_like(out.feat)
+    from oracle import fixture_dout
+    g = fixture_dout(dict(out=out.feat, dout_seed=4))
     out.feat.backward(g)
-    sd = {k: v.detach().numpy() for k, v in model.state_dict().items()}
     keep = ("embedding.stem.conv.weight", "enc.enc0.block0.cpe.0.weight", "enc.enc0.block1.attn.qkv.weight",
             "enc.enc1.down.proj.weight", "enc.enc2.block1.cpe.0.weight", "dec.dec0.block0.cpe.0.weight",
             "dec.dec0.up.proj_skip.0.weight", "dec.dec1.block1.attn.proj.weight")
     grads = {"grad::" + k: p.grad.numpy() for k, p in model.named_parameters() if k in keep}
     np.savez_compressed(os.path.join(OUT, "ptv3_tiny.npz"), coord=coord, grid_coord=grid, offset=offset, feat=feat.numpy(),
-                        out=out.feat.detach().numpy(), dout=g.numpy(), **{"sd::" + k: v for k, v in sd.items()}, **grads)
+                        out=out.feat.detach().numpy(), dout_seed=np.int64(4), sd_spec=spec, sd_seed=seed, **grads)
     print("ptv3_tiny.npz", out.feat.shape, float(out.feat.abs().mean()))
 
 
@@ -271,21 +282,74 @@ def gen_spunet_tiny():
     cfg = dict(in_channels=6, num_classes=13, base_channels=8, channels=(8, 16, 16, 24, 24, 16, 16, 8), layers=(2, 1, 1, 1, 1, 1, 1, 2))
     model = ref.spunet.SpUNetBase(**cfg)
     model.train()
-    with torch.no_grad():        # the reference initialises BatchNorm to (1, 0) and biases to 0: perturb so that every term is exercised
-        for k, p in model.named_parameters():
-            if p.dim() == 1:
-                p.add_(0.1 * torch.randn_like(p))
+    spec, seed = _seeded_weights(model, 5)   # 1-D parameters perturbed away from (1, 0) so that every term is exercised
     b = synth.make_batch(2, seed=21, target_voxels=1200)
     out = model(dict(grid_coord=torch.from_numpy(b["grid_coord"]), feat=torch.from_numpy(b["feat"]), offset=torch.from_numpy(b["offset"])))
     g = torch.randn_like(out)
     out.backward(g)
-    sd = {k: v.detach().numpy() for k, v in model.state_dict().items()}
     grads = {"grad::" + k: p.grad.numpy() for k, p in model.named_parameters()}
     np.savez_compressed(os.path.join(OUT, "spunet_tiny.npz"), grid_coord=b["grid_coord"], offset=b["offset"], feat=b["feat"],
                         out=out.detach().numpy(), dout=g.numpy(), layers=np.array(cfg["layers"]), channels=np.array(cfg["channels"]),
-                        **{"sd::" + k: v for k, v in sd.items()}, **grads)
+                        sd_spec=spec, sd_seed=seed, **grads)
     print("spunet_tiny.npz", out.shape, float(out.abs().mean()), len(grads), "parameter gradients")
 
+
+def gen_dropin_abi():
+    """reference_dropin.npz (one JSON string): parameter names / shapes of the reference's own PT-v3m1 (base config) and SpUNet-v1m1 (6 -> 20) built on
+    the drop-in spconv / flash_attn modules, and what the reference's Point.sparsify() makes of a seeded point set."""
+    import json
+    from pointcept_b200.ptv3 import ptv3_base_config
+    ref = ref_import.load_models(use_shims=True)
+    shapes = lambda m: [[k, list(v.shape)] for k, v in m.state_dict().items()]   # noqa: E731
+    g = torch.Generator().manual_seed(0)
+    grid = torch.randint(0, 50, (100, 3), generator=g)
+    feat = torch.randn(100, 6, generator=g)
+    pt = ref.structure.Point(grid_coord=grid, feat=feat, offset=torch.tensor([60, 100]))
+    pt.sparsify()
+    x = pt.sparse_conv_feat
+    out = dict(ptv3_base=shapes(ref.ptv3.PointTransformerV3(**ptv3_base_config())), spunet_6_20=shapes(ref.spunet.SpUNetBase(6, 20)),
+               sparsify=dict(grid_coord=grid.tolist(), offset=[60, 100], indices=x.indices.tolist(), spatial_shape=[int(v) for v in x.spatial_shape],
+                             batch_size=int(x.batch_size)))
+    np.savez_compressed(os.path.join(OUT, "reference_dropin.npz"), json=np.array(json.dumps(out, separators=(",", ":"))))
+    print("reference_dropin.npz", len(out["ptv3_base"]), len(out["spunet_6_20"]))
+
+
+def gen_collate():
+    """collate_fn.pt: the reference's own collate_fn (pointcept/datasets/utils.py:19-73) on the seeded CPU inputs of
+    tests/test_host_logic.py::test_collate_fn_matches_the_reference_function (torch.save of tensors, dicts, lists and strings)."""
+    import importlib.util
+    import types
+    saved = {k: sys.modules.get(k) for k in ("torch_scatter", "pointcept", "pointcept.models", "pointcept.models.utils")}
+    try:
+        sys.modules["torch_scatter"] = types.SimpleNamespace(scatter_min=None)
+        for name in ("pointcept", "pointcept.models"):
+            sys.modules[name] = types.ModuleType(name)
+        sys.modules["pointcept.models.utils"] = types.SimpleNamespace(offset2batch=None)
+        spec = importlib.util.spec_from_file_location("_ref_datasets_utils", os.path.join(ref_import.REF, "pointcept/datasets/utils.py"))
+        ref = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(ref)
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                sys.modules.pop(k, None)
+            else:
+                sys.modules[k] = v
+    sys.path.insert(0, os.path.join(os.path.dirname(OUT)))
+    from test_host_logic import collate_inputs
+    inp = collate_inputs()
+    strip = lambda d: {k: v for k, v in d.items() if k != "name"}     # noqa: E731  (the reference cannot re-collate lists of str)
+    two = [ref.collate_fn([strip(d) for d in inp["batch"][:2]]), ref.collate_fn([strip(d) for d in inp["batch"][1:]])]
+    out = dict(batch=ref.collate_fn([dict(d) for d in inp["batch"]]), two_in=two, two=ref.collate_fn([dict(d) for d in two]),
+               tensors=ref.collate_fn(list(inp["tensors"])), numbers=ref.collate_fn([[1, 2], [3]]), strings=ref.collate_fn(["a", "b"]))
+    torch.save(out, os.path.join(OUT, "collate_fn.pt"))
+    print("collate_fn.pt", sorted(out))
+
+
+if __name__ == "__main__" and "--only-dropin" in sys.argv:
+    assert ref_import.available(), "needs /root/reference"
+    gen_dropin_abi()
+    gen_collate()
+    sys.exit(0)
 
 if __name__ == "__main__" and "--only-spunet" in sys.argv:
     assert ref_import.available(), "needs /root/reference"
@@ -314,5 +378,7 @@ if __name__ == "__main__":
         gen_grid_sample()
         gen_point_rope()
         gen_spunet_tiny()
+        gen_dropin_abi()
+        gen_collate()
         gen_ptv3_tiny()
 

@@ -1,7 +1,7 @@
-"""BASELINE.md B2 comparator: the reference's GPU path for the same PT-v3m1 / SpUNet step on the same B200.
+"""BASELINE.md B2 comparator: the reference's GPU path for the same PT-v3m1 / SpUNet step on the same GPU.
 
-What the reference runs on a GPU is third-party: flash-attn 2.8.3 (present in this image, sm_100 cubins of its FA2 mma.sync
-kernels) and spconv (NOT installable offline; `profiles/r02_spconv_install_attempt.txt`).  This module re-wires the mirror models
+What the reference runs on a GPU is third-party: flash-attn 2.8.3 (when installed; the FA2 mma.sync
+kernels) and spconv (NOT installable offline: `pip install spconv-cu124 / -cu126` finds no matching distribution).  This module re-wires the mirror models
 of this repo onto that stack:
   * attention   -> stock ``flash_attn.flash_attn_varlen_qkvpacked_func`` (the exact call of ptv3m1:208-214)
   * sparse conv -> torch-native rulebook convolution, per kernel offset gather -> ``mm`` -> ``index_add_`` (spconv's "Native"
@@ -125,6 +125,6 @@ def reference_gpu_ops():
         _ptv3._FUSED_LOSS = saved_ptv3["loss"]
 
 
-DESCRIPTION = ("same step on the reference's GPU stack: stock flash-attn {fa} (FA2 mma.sync kernels, sm_100 cubin) for the patch "
+DESCRIPTION = ("same step on the reference's GPU stack: stock flash-attn {fa} (FA2 mma.sync kernels) for the patch "
                "attention, torch-native gather->mm->index_add_ rulebook convolution (spconv is not installable offline), torch "
                "LayerNorm/Linear/indexing glue; index-side tables from this repo's kernels in both arms")
